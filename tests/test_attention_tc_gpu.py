@@ -1,9 +1,12 @@
-"""wgmma flash-attention kernel vs an fp32 reference on the same bf16 inputs (LLaMA prefill and DINOv2 shapes, both
-operand layouts: KV cache [B,H,cap,D] and fused-qkv activation slices)."""
+"""wgmma flash-attention kernel at LLaMA prefill and DINOv2 shapes, both operand layouts (KV cache [B,H,cap,D] and
+fused-qkv activation slices): per element against the fp64 reference of tests/parity.py, and in agreement with the
+mma.sync kernel (ops.attention).  The edge cases of the tiling are in tests/test_attention_wgmma_gpu.py."""
 import math
 
 import pytest
 import torch
+
+from tests import parity as P
 
 pytestmark = pytest.mark.gpu
 
@@ -12,23 +15,17 @@ def rnd(*shape, seed=0):
     return torch.randn(*shape, generator=torch.Generator().manual_seed(seed))
 
 
-def ref_attn(q, k, v, causal, scale, q_pos0=0, kv_len=None):
-    B, Sq, H, D = q.shape
-    Sk = k.shape[2]
-    s = torch.einsum("bqhd,bhkd->bhqk", q.float(), k.float()) * scale
-    mask = torch.zeros(B, 1, Sq, Sk, dtype=torch.bool)
-    if causal:
-        mask |= (torch.arange(Sk)[None, :] > (torch.arange(Sq)[:, None] + q_pos0))[None, None]
-    if kv_len is not None:
-        mask |= (torch.arange(Sk)[None, :] >= kv_len[:, None])[:, None, None, :]
-    p = torch.softmax(s.masked_fill(mask, float("-inf")), -1)
-    return torch.einsum("bhqk,bhkd->bqhd", p, v.float()).reshape(B, Sq, H * D)
+def check(got, q, k, v, what, *, causal, scale, q_pos0=0, kv_len=None):
+    ref, pv = P.attention_ref(q.cuda(), k.cuda(), v.cuda(), causal=causal, scale=scale, q_pos0=q_pos0,
+                              kv_len=None if kv_len is None else kv_len.cuda())
+    P.check_attention(got, ref, pv, what=what)
+    return ref
 
 
 @pytest.mark.parametrize("B,H,S,D,causal", [(1, 1, 128, 128, False), (1, 1, 128, 64, False), (2, 3, 200, 128, True), (2, 2, 1025, 64, False),
                                             (1, 2, 966, 128, True), (3, 2, 70, 64, True),
-                                            # key / query remainders that take the tail paths (<= 8 trailing keys merged in the epilogue,
-                                            # <= 16 trailing query rows on the mma.sync kernel) and their first non-tail neighbours
+                                            # S = 1027, 260, 5, 136, 137, 528, 529, 1025: a ragged last key tile of 3, 4, 5, 8, 9, 16,
+                                            # 17 or 1 keys and a last query tile of as many rows (warpgroup 1 idle); 1025 causal: 9 tiles
                                             (2, 2, 1027, 128, False), (2, 3, 260, 64, False), (1, 2, 5, 64, False), (2, 1, 136, 128, False),
                                             (1, 2, 137, 64, False), (1, 2, 528, 64, False), (1, 1, 529, 128, False), (2, 2, 1025, 64, True)])
 def test_attention_tc_cache_layout(B, H, S, D, causal):
@@ -38,14 +35,11 @@ def test_attention_tc_cache_layout(B, H, S, D, causal):
     kc = torch.zeros(B, H, cap, D, dtype=torch.bfloat16); vc = torch.zeros_like(kc)
     kc[:, :, :S] = rnd(B, H, S, D, seed=2).bfloat16(); vc[:, :, :S] = rnd(B, H, S, D, seed=3).bfloat16()
     scale = 1.0 / math.sqrt(D)
-    want = ref_attn(q, kc[:, :, :S], vc[:, :, :S], causal, scale)
-    got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=causal, scale=scale, sk=S).float().cpu()
-    err = ((got - want).abs().max() / want.abs().max()).item()
-    print(f"B={B} H={H} S={S} D={D} causal={causal}: norm-rel err {err:.2e}")
-    assert err < 1e-2
+    got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=causal, scale=scale, sk=S)
+    ref = check(got, q, kc[:, :, :S], vc[:, :, :S], f"B={B} H={H} S={S} D={D} causal={causal}", causal=causal, scale=scale)
     # agrees with the mma.sync kernel too
-    old = G.attention(q.cuda(), kc.cuda(), vc.cuda(), causal=causal, scale=scale, sk=S).float().cpu()
-    assert ((got - old).abs().max() / want.abs().max()).item() < 1e-2
+    old = G.attention(q.cuda(), kc.cuda(), vc.cuda(), causal=causal, scale=scale, sk=S)
+    assert ((got.double() - old.double()).abs().max() / ref.abs().max()).item() < 1e-2
 
 
 def test_attention_tc_qkv_layout_and_kvlen():
@@ -54,39 +48,29 @@ def test_attention_tc_qkv_layout_and_kvlen():
     qkv = rnd(B, S, 3 * H * D, seed=4).bfloat16()
     x = qkv.cuda().reshape(B, S, 3, H, D)
     q, k, v = x[:, :, 0], x[:, :, 1].permute(0, 2, 1, 3), x[:, :, 2].permute(0, 2, 1, 3)
-    kv_len = torch.tensor([300, 111], dtype=torch.int32)
-    got = G.attention_tc(q, k, v, causal=False, scale=0.125, kv_len=kv_len.cuda()).float().cpu()
-    xc = qkv.reshape(B, S, 3, H, D)
-    want = ref_attn(xc[:, :, 0], xc[:, :, 1].permute(0, 2, 1, 3), xc[:, :, 2].permute(0, 2, 1, 3), False, 0.125, 0, kv_len.long())
-    assert ((got - want).abs().max() / want.abs().max()).item() < 1e-2
-    # ragged non-causal lengths: one row ends 2 keys past a full tile (tail path), one does not
-    kv_len = torch.tensor([258, 300], dtype=torch.int32)
-    got = G.attention_tc(q, k, v, causal=False, scale=0.125, kv_len=kv_len.cuda()).float().cpu()
-    want = ref_attn(xc[:, :, 0], xc[:, :, 1].permute(0, 2, 1, 3), xc[:, :, 2].permute(0, 2, 1, 3), False, 0.125, 0, kv_len.long())
-    assert ((got - want).abs().max() / want.abs().max()).item() < 1e-2
+    # one sequence ends inside key tile 0; then one ends 2 keys into key tile 2 (rows 256, 257)
+    for lens in ([300, 111], [258, 300]):
+        kv_len = torch.tensor(lens, dtype=torch.int32)
+        got = G.attention_tc(q, k, v, causal=False, scale=0.125, kv_len=kv_len.cuda())
+        check(got, q, k, v, f"qkv layout kv_len={lens}", causal=False, scale=0.125, kv_len=kv_len)
     # causal + kv_len + right-padded rows (LLaMA prefill semantics): rows beyond kv_len still produce finite output
     B, S, H, D = 2, 190, 2, 128
     q = rnd(B, S, H, D, seed=5).bfloat16(); kc = rnd(B, H, 256, D, seed=6).bfloat16(); vc = rnd(B, H, 256, D, seed=7).bfloat16()
     kv_len = torch.tensor([190, 60], dtype=torch.int32)
-    got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=True, scale=0.088, kv_len=kv_len.cuda(), sk=S).float().cpu()
-    want = ref_attn(q, kc[:, :, :S], vc[:, :, :S], True, 0.088, 0, kv_len.long())
+    got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=True, scale=0.088, kv_len=kv_len.cuda(), sk=S)
     assert torch.isfinite(got).all()
-    assert ((got - want).abs().max() / want.abs().max()).item() < 1e-2
+    check(got, q, kc[:, :, :S], vc[:, :, :S], "causal kv_len=[190, 60]", causal=True, scale=0.088, kv_len=kv_len)
 
 
 def test_attention_tc_query_tail_row_with_ragged_kv():
-    """Sq = 2 * 256 + 1, D = 64, non-causal: the last query row runs on the producer warpgroup's idle warps (q_tail) out of the
-    shared-memory K / V ring.  Ragged kv_len exercises its masking (a partly valid last tile), the trailing-key merge (kv_len 2
-    past a full tile) and a row with fewer keys than one tile."""
+    """Sq = 4 * 128 + 1, D = 64, non-causal: the last query tile holds one row (warpgroup 1 wholly past Sq).  Ragged kv_len:
+    a partly valid last key tile, 2 keys into a tile (258), a length shorter than one tile (7), exactly four tiles (512)."""
     from groma_b200 import ops as G
     B, S, H, D = 4, 513, 2, 64
     q = rnd(B, S, H, D, seed=21).bfloat16(); kc = rnd(B, H, S, D, seed=22).bfloat16(); vc = rnd(B, H, S, D, seed=23).bfloat16()
     for lens in ([513, 130, 258, 7], [513, 513, 512, 385]):
         kv_len = torch.tensor(lens, dtype=torch.int32)
-        got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=False, scale=0.125, kv_len=kv_len.cuda(), sk=S).float().cpu()
-        want = ref_attn(q, kc, vc, False, 0.125, 0, kv_len.long())
+        got = G.attention_tc(q.cuda(), kc.cuda(), vc.cuda(), causal=False, scale=0.125, kv_len=kv_len.cuda(), sk=S)
         assert torch.isfinite(got).all()
-        err_all = ((got - want).abs().max() / want.abs().max()).item()
-        err_tail = ((got[:, -1] - want[:, -1]).abs().max() / want.abs().max()).item()
-        print(f"kv_len {lens}: norm-rel err {err_all:.2e}, tail row {err_tail:.2e}")
-        assert err_all < 1e-2 and err_tail < 1e-2
+        check(got, q, kc, vc, f"Sq=513 kv_len={lens}", causal=False, scale=0.125, kv_len=kv_len)
+        check(got[:, -1:], q[:, -1:], kc, vc, f"Sq=513 kv_len={lens} last row", causal=False, scale=0.125, kv_len=kv_len)
