@@ -313,6 +313,48 @@ def beam_denominators(length_penalty: float, max_length: int) -> torch.Tensor:
     return torch.tensor([float(n) ** float(length_penalty) if n > 0 else 1.0 for n in range(max_length + 1)], dtype=torch.float64)
 
 
+def resolve_prompt_groups(rows: int, n_images: int, refer_boxes=None, ground_boxes=None, kv_cache_dtype=torch.bfloat16,
+                          num_beams=None) -> int:
+    """n, the prompts per image of a generate(input_ids [rows, L], images [n_images, ...]) call: rows b*n .. b*n + n - 1 ask
+    about image b, whose vision stage, region selection and shared prompt prefix run once (DESIGN.md section 4).  1 when
+    rows == n_images (the plain call).  Raises ValueError when rows is not a multiple of n_images, and for n > 1 with refer /
+    ground boxes (they change the region set per row), with an fp8 KV cache, with n > ops.GROUP_MAX_PROMPTS or with rows above
+    ops.BEAM_MAX_ROWS; NotImplementedError for num_beams > 1 with n > 1."""
+    if n_images < 1 or rows % n_images != 0:
+        raise ValueError(f"input_ids has {rows} rows, which is not a multiple of the {n_images} images: the rows b*n .. b*n+n-1 "
+                         "of a grouped generate() ask about image b")
+    n = rows // n_images
+    if n == 1:
+        return 1
+    if num_beams is not None and not isinstance(num_beams, bool) and isinstance(num_beams, (int, np.integer)) and num_beams > 1:
+        raise NotImplementedError("num_beams > 1 with several prompts per image is not implemented; pass one row per image")
+    if refer_boxes is not None or ground_boxes is not None:
+        raise ValueError("refer_boxes / ground_boxes cannot be combined with several prompts per image: they change the region "
+                         "set of each row, so the rows share nothing; pass one row per image")
+    if kv_cache_dtype == torch.float8_e4m3fn:
+        raise ValueError("several prompts per image need a bf16 KV cache; set model.kv_cache_dtype = torch.bfloat16")
+    if n > G.GROUP_MAX_PROMPTS:
+        raise ValueError(f"{n} prompts per image exceed the grouped decode attention's limit of {G.GROUP_MAX_PROMPTS}")
+    if rows > G.BEAM_MAX_ROWS:
+        raise ValueError(f"{rows} rows exceed the {G.BEAM_MAX_ROWS} rows of the decode GEMMs")
+    return n
+
+
+def rows_of_images(per_image: Sequence, n: int) -> list:
+    """Row i of a grouped call takes image i // n's entry."""
+    return [x for x in per_image for _ in range(n)]
+
+
+def shared_prefix_len(ids: torch.Tensor, n: int) -> int:
+    """P of a grouped generate(): over the assembled rows ids [B*n, T] (rows of an image consecutive), the minimum over images of
+    the longest common prefix of that image's n rows, capped at T - 1 so that every row keeps at least one position of its
+    own (the one whose logits give its first token)."""
+    R, T = ids.shape
+    g = ids.reshape(R // n, n, T)
+    agree = (g == g[:, :1]).all(1).all(0)
+    return min(int(agree.long().cumprod(0).sum()), T - 1)
+
+
 def _c2c(b: torch.Tensor) -> torch.Tensor:
     return torch.cat([b[:, :2] - 0.5 * b[:, 2:], b[:, :2] + 0.5 * b[:, 2:]], -1)
 
@@ -584,7 +626,9 @@ class GromaModel(torch.nn.Module):
 
     # ------------------------------------------------------------------ vision + splice (groma.py:219-375)
     @torch.no_grad()
-    def _prefill_inputs(self, input_ids, images, refer_boxes, ground_boxes, labels=None, selected_override=None):
+    def _prefill_inputs(self, input_ids, images, refer_boxes, ground_boxes, labels=None, selected_override=None, n: int = 1):
+        """n > 1: rows b*n .. b*n + n - 1 of input_ids ask about image b (resolve_prompt_groups); the vision stage and the
+        selection run per image, and each row is assembled with its image's image and region tokens."""
         eng, cfg = self.engine, self.config
         dev = eng.dev
         self._mark("start")
@@ -614,13 +658,16 @@ class GromaModel(torch.nn.Module):
         else:
             selected = eng.select_regions(pc, px, sc, refer_boxes, ground_boxes, cfg.nms_thres, cfg.box_score_thres, cfg.max_region_num,
                                           overlap=_queue_maps)
+        sel_img = selected
+        if n > 1:
+            selected = rows_of_images(sel_img, n)
         refer_inds = self._match(ids_h, labels_h, selected, refer_boxes, ground_boxes)
         if not torch.equal(ids_h, ids_h0):
             input_ids.copy_(ids_h.to(input_ids.device))           # the reference edits the caller's tensor in place (T8)
             if labels is not None:
                 labels.copy_(labels_h.to(labels.device))
         self._mark("select+maps")
-        region = eng.region_tokens(maps["xs"], selected)
+        region = eng.region_tokens(maps["xs"], sel_img)
         self._mark("region_tokens")
         counts = [len(b) for b in selected]
         ids_new, labels_new = self._assemble(ids_h, labels_h, counts, img_tok.shape[1])
@@ -629,16 +676,25 @@ class GromaModel(torch.nn.Module):
         flat = ids_new.reshape(-1)
         img_pos = (flat == self.img_token_id).nonzero(as_tuple=True)[0]
         reg_pos = (flat == self.reg_token_id).nonzero(as_tuple=True)[0]
-        G.scatter_rows(img_pos.to(dev), img_tok.reshape(-1, x.shape[-1]), x)
+        img_src, reg_src = img_tok.reshape(-1, x.shape[-1]), region
+        if n > 1:
+            # row i takes image i // n's tokens: gather the per-image rows into per-row order
+            n_img = img_tok.shape[1]
+            offs = np.cumsum([0] + [len(b) for b in sel_img])
+            img_idx = torch.cat([torch.arange(n_img) + (i // n) * n_img for i in range(Bn)])
+            reg_idx = torch.cat([torch.arange(offs[i // n], offs[i // n + 1]) for i in range(Bn)])
+            img_src = G.gather_rows(img_idx.to(dev).contiguous(), img_src)
+            reg_src = G.gather_rows(reg_idx.to(dev).contiguous(), region) if len(reg_idx) > 0 else region
+        G.scatter_rows(img_pos.to(dev), img_src, x)
         if len(reg_pos) > 0:
-            G.scatter_rows(reg_pos.to(dev), region, x)
+            G.scatter_rows(reg_pos.to(dev), reg_src, x)
         ref_pos = (flat == self.refer_feat_token_id).nonzero(as_tuple=True)[0]
         if len(ref_pos) > 0:
             offs, o = [], 0
             for c, ind in zip(counts, refer_inds):
                 offs.append(ind + o)
                 o += c
-            src = G.gather_rows(torch.cat(offs).to(dev).contiguous(), region)
+            src = G.gather_rows(torch.cat(offs).to(dev).contiguous(), reg_src)
             G.scatter_rows(ref_pos.to(dev), src, x)
         attn_mask = ids_new.ne(self.pad_token_id)
         vis_outputs = {"pred_boxes": [b.to(dev) for b in selected], "image_features": img_tok, "region_features": region}
@@ -666,6 +722,8 @@ class GromaModel(torch.nn.Module):
         eng = self.engine
         vis_outputs = None
         if past_key_values is None:
+            if eng.drop_group():          # a prefill replaces the caches of an earlier grouped generate()
+                self._graph = None
             x, ids_new, labels_new, mask, vis_outputs, aux = self._prefill_inputs(input_ids, images, refer_boxes, ground_boxes, labels,
                                                                                   _selected_override)
             B, T = ids_new.shape
@@ -738,7 +796,11 @@ class GromaModel(torch.nn.Module):
         length_penalty, early_stopping and num_return_sequences (resolve_beam_params, oracle/beam_search.py): `sequences` is
         [B * num_return_sequences, L] with the rows of an image consecutive and GenerateOutput.sequences_scores is set.  The
         vision stage and the prefill run once per image, so hidden_states keeps one (None, vis_outputs) whose pred_boxes has B
-        entries, and past_key_values is None (4.32's BeamSearchDecoderOnlyOutput)."""
+        entries, and past_key_values is None (4.32's BeamSearchDecoderOnlyOutput).
+        input_ids with n >= 2 rows per image (resolve_prompt_groups): rows b*n .. b*n + n - 1 ask about image b, and the result
+        is that of the same rows on images.repeat_interleave(n, 0) with each image's selection repeated per row.  The vision
+        stage and selection run once per image, the prefix the rows of an image share is prefilled once, and the decode
+        attention reads it once per image (engine.group_buffers); pred_boxes has B*n entries and past_key_values is None."""
         sampling = do_sample is True
         gc = generation_config or self.generation_config
         if sampling:
@@ -746,6 +808,11 @@ class GromaModel(torch.nn.Module):
         if max_new_tokens is None:
             max_new_tokens = getattr(gc, "max_new_tokens", None) or 20
         eos_ids = _eos_list(eos_token_id if eos_token_id is not None else getattr(gc, "eos_token_id", None))
+        n_grp = 1 if images is None else resolve_prompt_groups(input_ids.shape[0], images.shape[0], refer_boxes, ground_boxes,
+                                                                self.engine.kv_dtype, num_beams)
+        if n_grp > 1 and _selected_override is not None and len(_selected_override) != images.shape[0]:
+            raise ValueError(f"_selected_override of a grouped call holds one selection per image ({images.shape[0]}), "
+                             f"got {len(_selected_override)}")
         beam = resolve_beam_params(gc, num_beams, length_penalty, early_stopping, num_return_sequences, input_ids.shape[0], do_sample,
                                    self.engine.kv_dtype, eos_ids, **kwargs)
         pad_id = getattr(gc, "pad_token_id", None)
@@ -763,14 +830,26 @@ class GromaModel(torch.nn.Module):
         eng.kv_mirror, eng.kv_mirror_len = None, 0     # fp8: generate() hands out one dequantised copy at the end
         if eng.drop_beam():                            # a greedy call frees the beam cache of an earlier beam search
             self._graph = None                         # (and the beam graph that addressed it)
-        x, ids_new, _, mask, vis_outputs, aux = self._prefill_inputs(input_ids, images, refer_boxes, ground_boxes, None, _selected_override)
+        if n_grp == 1 and eng.drop_group():            # and the caches of an earlier grouped call
+            self._graph = None
+        x, ids_new, _, mask, vis_outputs, aux = self._prefill_inputs(input_ids, images, refer_boxes, ground_boxes, None, _selected_override,
+                                                                     n=n_grp)
         B, T = ids_new.shape
         eng.ensure_rope(T + max_new_tokens)        # HF's rotary cache extends on demand; ours is rebuilt before the kernels index it
-        eng.alloc_kv(B, T + max_new_tokens)
+        group = None
+        if n_grp == 1:
+            eng.alloc_kv(B, T + max_new_tokens)
+        else:
+            # prompt groups: shared prefix + per-row caches (engine.group_buffers); no per-row cache of the whole prompt exists
+            eng.drop_kv()
+            group = eng.group_buffers(B // n_grp, n_grp, shared_prefix_len(ids_new, n_grp), T, max_new_tokens)
         kv_len = mask.sum(1).to(torch.int32).to(dev)
         self._last = dict(ids=ids_new, mask=mask, aux=aux)
         self._mark("assemble+embed")
-        logits = eng.llm_prefill(x, B, T, kv_len, last_only=True)          # [B, V] at the last (padded) position
+        if group is None:
+            logits = eng.llm_prefill(x, B, T, kv_len, last_only=True)          # [B, V] at the last (padded) position
+        else:
+            logits = eng.llm_prefill_grouped(x, group, T, kv_len)
         self._mark("llm_prefill")
         d = eng._decode_buffers(B)
         if process:
@@ -805,18 +884,19 @@ class GromaModel(torch.nn.Module):
                 if bool(torch.isin(out_tokens[:steps_done], eos_t).any(0).all()):
                     break
             if self.use_cuda_graph and graph is None and s >= 2:
-                graph = self._capture(B, sample=sampling, process=process)
+                graph = self._capture(B, sample=sampling, process=process, group=group)
             if graph is not None:
                 graph.replay()
             else:
-                eng.decode_step(B, sample=sampling, process=process)
+                eng.decode_step(B, sample=sampling, process=process, group=group)
             out_tokens[s].copy_(d["ids"])
             if self._step_logits is not None:
                 self._step_logits.append(d["logits"].clone())
             steps_done = s + 1
         self._mark("decode")
         eng.check_decode_status()
-        eng.past = T + steps_done - 1
+        # a grouped call hands out no cache: forward(past_key_values=...) must start from a prefill
+        eng.past = T + steps_done - 1 if group is None else -1
         new = out_tokens[:steps_done].t().contiguous()
         if eos_t is not None:
             # HF greedy_search semantics: a row that has emitted EOS is fed / reported as pad_token_id from then on, and
@@ -832,7 +912,7 @@ class GromaModel(torch.nn.Module):
         if not return_dict_in_generate:
             return sequences
         return GenerateOutput(sequences=sequences, hidden_states=((None, vis_outputs),) if output_hidden_states else (),
-                              past_key_values=self._kv_tuple(eng.past) if use_cache else None)
+                              past_key_values=self._kv_tuple(eng.past) if use_cache and group is None else None)
 
     def _generate_beam(self, input_ids, images, refer_boxes, ground_boxes, max_new_tokens, eos_ids, pad_id, proc, beam,
                        return_dict_in_generate, output_hidden_states, _selected_override, keep_logits):
@@ -844,6 +924,8 @@ class GromaModel(torch.nn.Module):
         if pad_id is None:
             pad_id = self.pad_token_id if self.pad_token_id is not None else (eos_ids[0] if eos_ids else 0)
         eng.kv_mirror, eng.kv_mirror_len = None, 0
+        if eng.drop_group():
+            self._graph = None
         x, ids_new, _, mask, vis_outputs, aux = self._prefill_inputs(input_ids, images, refer_boxes, ground_boxes, None, _selected_override)
         B, T = ids_new.shape
         R, L0 = B * nb, input_ids.shape[1]
@@ -899,18 +981,20 @@ class GromaModel(torch.nn.Module):
         return GenerateOutput(sequences=sequences, hidden_states=((None, vis_outputs),) if output_hidden_states else (),
                               past_key_values=None, sequences_scores=torch.tensor(scores, dtype=torch.float32).to(dev))
 
-    def _capture(self, B: int, sample: bool = False, process: bool = False, beam: Optional[dict] = None):
+    def _capture(self, B: int, sample: bool = False, process: bool = False, beam: Optional[dict] = None, group: Optional[dict] = None):
         """Capture one decode step (all 32 layers + heads + [logits processors] + argmax or sampling + position advance) into a
         CUDA graph.  Sampling and processing read their parameters, seed and token history from device buffers, so one graph
         serves every setting whose buffers fit (the buffers' addresses are part of the key)."""
         eng = self.engine
         d = eng._decode_buffers(B)
-        key = (B, eng.kv.data_ptr(), eng.kv_cap, eng.rope_cos.data_ptr(), eng.use_megakernel, eng.kv_dtype,
+        key = (B, eng.kv.data_ptr() if eng.kv is not None else 0, getattr(eng, "kv_cap", 0), eng.rope_cos.data_ptr(), eng.use_megakernel, eng.kv_dtype,
                eng.kv_scale.data_ptr() if eng.kv_scale is not None else 0, sample, process)
         if process:
             key += (d["hist"].data_ptr(), d["hist"].shape[1], d["proc_params"].data_ptr(), d["proc_params"].numel())
         if beam is not None:
             key += ("beam", beam["nb"], beam["kv"].data_ptr(), beam["src"].shape[1], beam["hist"].shape[1], beam["denom"].data_ptr())
+        if group is not None:
+            key += ("group", group["n"], group["P"], group["prefix"].data_ptr(), group["row"].data_ptr(), group["row"].shape[4])
         if self._graph is not None and self._graph[0] == key:
             return self._graph[1]
         g = torch.cuda.CUDAGraph()
@@ -921,7 +1005,7 @@ class GromaModel(torch.nn.Module):
         with torch.cuda.stream(s):
             # thread_local: NCCL's watchdog thread may touch the CUDA API while this thread captures
             with torch.cuda.graph(g, stream=s, capture_error_mode="thread_local"):
-                eng.decode_step(B, sample=sample, process=process, beam=beam)
+                eng.decode_step(B, sample=sample, process=process, beam=beam, group=group)
         self._graph_kernels = G.LAUNCHES - l0
         torch.cuda.current_stream().wait_stream(s)
         for k, v in saved.items():      # capture does not execute; restore just in case of warm-up side effects

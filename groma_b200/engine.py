@@ -767,8 +767,14 @@ class GromaEngine:
         self.kv, self.kv_scale, self.kv_cap = new, new_sc, cap
 
     def kv_bytes(self) -> int:
-        """Device bytes of the KV cache: bf16 rows, or fp8 codes + fp32 scales."""
-        return self.kv.numel() * self.kv.element_size() + (self.kv_scale.numel() * 4 if self.kv_scale is not None else 0)
+        """Device bytes of the KV caches: bf16 rows, or fp8 codes + fp32 scales, plus the prefix and row caches of a grouped
+        generate() (group_buffers) while they are held."""
+        n = 0 if self.kv is None else self.kv.numel() * self.kv.element_size()
+        n += self.kv_scale.numel() * 4 if self.kv_scale is not None else 0
+        g = getattr(self, "_group", None)
+        if g is not None:
+            n += (g["prefix"].numel() + g["row"].numel()) * 2
+        return n
 
     def kv_layer(self, i: int):
         """(k, v, k scales, v scales) of layer i; the scales are None for a bf16 cache."""
@@ -801,6 +807,29 @@ class GromaEngine:
     def llm_prefill(self, x: torch.Tensor, B: int, T: int, kv_len: torch.Tensor, last_only: bool = False) -> torch.Tensor:
         """$HF/models/llama/modeling_llama.py LlamaModel forward (32 x LlamaDecoderLayer :292-340) + both heads
         (groma.py:399-402).  x [B*T, hidden] bf16 (consumed), kv_len int32 [B] = valid (non-pad) length per row."""
+        cfg = self.cfg
+        nh, hd = cfg.llm_heads, cfg.head_dim
+        if self.kv_fp8:
+            # the prefill attends over the bf16 K/V it computes (a per-layer staging buffer); groma_kv_quantize then writes them
+            # into the fp8 cache
+            stage = torch.empty((2, B, nh, T, hd), dtype=torch.bfloat16, device=self.dev)
+            self._prefill_layers(x, B, T, kv_len, lambda i: (stage[0], stage[1]),
+                                 written=lambda i: G.kv_quantize(stage, self.kv[i], self.kv_scale[i]))
+        else:
+            self._prefill_layers(x, B, T, kv_len, lambda i: (self.kv[i, 0], self.kv[i, 1]))
+        self.past = T
+        return self._prefill_head(x, B, T, last_only)
+
+    def _prefill_head(self, x: torch.Tensor, B: int, T: int, last_only: bool) -> torch.Tensor:
+        if last_only:
+            x = x.reshape(B, T, -1)[:, -1].contiguous()
+        h = G.rmsnorm(x, self.w["llm.norm"], self.cfg.rms_eps)
+        return G.gemm(h, self._wp("head.w"), out_f32=True)
+
+    def _prefill_layers(self, x: torch.Tensor, B: int, T: int, kv_len: torch.Tensor, kv_at, pos0: int = 0, written=None):
+        """The decoder layers over x [B*T, hidden] (updated in place) at positions pos0 .. pos0 + T - 1.  kv_at(i) gives layer i's
+        (k, v) [B, H, >= pos0 + T, D]: the rotated K/V are written at pos0 + t and the queries attend causally over positions
+        [0, pos0 + T) of it, keys at or past kv_len[b] masked.  written(i), if given, runs after layer i's attention."""
         cfg, w = self.cfg, self.w
         nh, hd = cfg.llm_heads, cfg.head_dim
         q = torch.empty((B * T, nh * hd), dtype=torch.bfloat16, device=self.dev)
@@ -811,32 +840,79 @@ class GromaEngine:
         # applies: head_dim 128 and enough rows to fill the SMs; tiny test configs keep gemm + rope_kv (same values)
         # (fp8 weights: no fused form -- two accumulator sets do not fit the 256-wide tile's registers)
         fused_rope = self.use_fused_rope and hd == 128 and nh % 2 == 0 and (bn2 == 512 or B * T >= 1024) and not self.fp8
-        if self.kv_fp8:
-            # the prefill attends over the bf16 K/V it computes (a per-layer staging buffer); groma_kv_quantize then writes them
-            # into the fp8 cache
-            stage = torch.empty((2, B, nh, T, hd), dtype=torch.bfloat16, device=self.dev)
         for i in range(cfg.llm_layers):
             o = f"llm.{i}."
             y = G.rmsnorm(x, w[o + "ln1"], cfg.rms_eps)
-            kc, vc = (stage[0], stage[1]) if self.kv_fp8 else (self.kv[i, 0], self.kv[i, 1])
+            kc, vc = kv_at(i)
             if fused_rope:
-                G.gemm_qkv_rope(y, self._wp(o + "qkv.w"), q, kc, vc, self.rope_cos, self.rope_sin, B, T, nh, hd, 0, block_n=bn2 or 256)
+                G.gemm_qkv_rope(y, self._wp(o + "qkv.w"), q, kc, vc, self.rope_cos, self.rope_sin, B, T, nh, hd, pos0,
+                                block_n=bn2 or 256)
             else:
                 qkv = self._proj(y, o + "qkv.w", block_n=bn2)
-                G.rope_kv(qkv, q, kc, vc, self.rope_cos, self.rope_sin, B, T, nh, hd, 0)
+                G.rope_kv(qkv, q, kc, vc, self.rope_cos, self.rope_sin, B, T, nh, hd, pos0)
             attn = G.attention_tc if (self.use_tc_attention and hd in (64, 128)) else G.attention
-            a = attn(q.reshape(B, T, nh, hd), kc, vc, causal=True, scale=1.0 / math.sqrt(hd), kv_len=kv_len, sk=T)
-            if self.kv_fp8:
-                G.kv_quantize(stage, self.kv[i], self.kv_scale[i])
+            a = attn(q.reshape(B, T, nh, hd), kc, vc, causal=True, scale=1.0 / math.sqrt(hd), q_pos0=pos0, kv_len=kv_len,
+                     sk=pos0 + T)
+            if written is not None:
+                written(i)
             self._proj(a.reshape(B * T, nh * hd), o + "o.w", residual=x, out=x, block_n=bn2)
             y = G.rmsnorm(x, w[o + "ln2"], cfg.rms_eps)
             gu = self._proj(y, o + "gu.w", act=G.ACT_SWIGLU)
             self._proj(gu, o + "down.w", residual=x, out=x, block_n=bn2)
+
+    # ------------------------------------------------------------------------------------------ prompt groups
+    def group_buffers(self, B: int, n: int, P: int, T: int, max_new: int):
+        """Caches of a grouped generate() over B images x n prompts (decode_step(group=...), include/groma_b200.h:
+        groma_decode_rope_attention_grouped): prefix [layer, k/v, B, H, P, D], the K/V of the P positions the rows of an image
+        share, and row [layer, k/v, B*n, H, T - P + max_new, D], each row's own positions (position p at index p - P), both
+        bf16.  They live apart from the plain cache `kv`; kept while the shapes are unchanged, so that a captured grouped step
+        stays valid across calls; a plain or beam generate() frees them (drop_group)."""
+        cfg = self.cfg
+        L, H, D = cfg.llm_layers, cfg.llm_heads, cfg.head_dim
+        rcap = T - P + max_new
+        st = getattr(self, "_group", None)
+        if st is not None and (st["B"], st["n"], st["P"], st["row"].shape[4]) == (B, n, P, rcap):
+            return st
+        self._group = st = None
+        with torch.inference_mode(False):
+            st = dict(B=B, n=n, P=P,
+                      prefix=torch.zeros((L, 2, B, H, P, D), dtype=torch.bfloat16, device=self.dev),
+                      row=torch.zeros((L, 2, B * n, H, rcap, D), dtype=torch.bfloat16, device=self.dev))
+        self._group = st
+        return st
+
+    def drop_group(self) -> bool:
+        """Free the caches of a grouped generate(); True if there were any."""
+        had = getattr(self, "_group", None) is not None
+        self._group = None
+        return had
+
+    def llm_prefill_grouped(self, x: torch.Tensor, st: dict, T: int, kv_len: torch.Tensor) -> torch.Tensor:
+        """The prefill of B images x n prompts whose assembled rows (x [B*n*T, hidden], rows of an image consecutive) agree on
+        their first P = st['P'] positions: the first row of each image runs positions [0, P) into st['prefix']; then every row
+        runs [P, T), attending to its image's prefix and its own positions through a per-layer staging buffer [B*n, H, T, D],
+        whose positions [P, T) go to st['row'].  kv_len int32 [B*n].  Returns fp32 logits [B*n, V] at the last position."""
+        cfg = self.cfg
+        B, n, P = st["B"], st["n"], st["P"]
+        R, nh, hd = B * n, cfg.llm_heads, cfg.head_dim
+        xr = x.view(B, n, T, -1)
+        if P > 0:
+            xp = xr[:, 0, :P].reshape(B * P, -1).contiguous()
+            kvl = kv_len.view(B, n)[:, 0].contiguous()
+            self._prefill_layers(xp, B, P, kvl, lambda i: (st["prefix"][i, 0], st["prefix"][i, 1]))
+        xs = xr[:, :, P:].reshape(R * (T - P), -1).contiguous()
+        stage = torch.empty((2, R, nh, T, hd), dtype=torch.bfloat16, device=self.dev)
+
+        def kv_at(i):
+            if P > 0:
+                stage.view(2, B, n, nh, T, hd)[:, :, :, :, :P].copy_(st["prefix"][i].unsqueeze(2))
+            return stage[0], stage[1]
+
+        def written(i):
+            st["row"][i][:, :, :, :T - P].copy_(stage[:, :, :, P:])
+        self._prefill_layers(xs, R, T - P, kv_len, kv_at, pos0=P, written=written)
         self.past = T
-        if last_only:
-            x = x.reshape(B, T, -1)[:, -1].contiguous()
-        h = G.rmsnorm(x, w["llm.norm"], cfg.rms_eps)
-        return G.gemm(h, self._wp("head.w"), out_f32=True)
+        return self._prefill_head(xs, R, T - P, last_only=True)
 
     def _decode_buffers(self, B: int):
         cfg = self.cfg
@@ -1123,7 +1199,8 @@ class GromaEngine:
         if process:
             G.history_append(d["hist"], d["hist_len"], d["ids"])
 
-    def decode_step(self, B: int, sample: bool = False, process: bool = False, beam: Optional[dict] = None) -> torch.Tensor:
+    def decode_step(self, B: int, sample: bool = False, process: bool = False, beam: Optional[dict] = None,
+                    group: Optional[dict] = None) -> torch.Tensor:
         """One greedy decode step for the whole batch (groma.py:376-402 + HF greedy argmax): reads d['ids'], appends K/V at
         *pos, attends to all kv_len[b] cached positions (all-ones mask, T7), writes next ids back to d['ids'].
         Every shape-dependent scalar lives on the device, so the step is CUDA-graph capturable.
@@ -1134,13 +1211,17 @@ class GromaEngine:
         process=True (generate()'s logits processors, state from process_buffers()): head reduce -> groma_logits_process ->
         argmax or groma_sample_tokens_ex -> history append -> advance; like sampling, it never takes the persistent kernel.
         beam (the state of beam_buffers()): B = images x beams rows; the attention is groma_decode_attention_beam over the prompt
-        cache and the beam cache, and the tail is head reduce -> beam_tail -> advance."""
+        cache and the beam cache, and the tail is head reduce -> beam_tail -> advance.
+        group (the caches of group_buffers()): B = images x n prompts rows; the attention is groma_decode_rope_attention_grouped
+        over the image's shared prefix and the row's own positions; the rest of the step is the plain one."""
         if (self.use_megakernel and self.mega_supported(B) and not sample and not process and not self.nf4 and not self.kv_fp8
-                and not self.fp8 and beam is None):
+                and not self.fp8 and beam is None and group is None):
             return self.decode_step_mega(B)
         if not self.fused_decode:
             if beam is not None:
                 raise G._lib.GromaError("the unfused decode step has no beam form")
+            if group is not None:
+                raise G._lib.GromaError("the unfused decode step has no prompt-group form")
             return self._decode_step_unfused(B, sample, process)
         cfg, w = self.cfg, self.w
         d = self._decode_buffers(B)
@@ -1192,9 +1273,13 @@ class GromaEngine:
 
         for i in range(cfg.llm_layers):
             o = f"llm.{i}."
-            kc, vc, ks, vs = self.kv_layer(i)
+            kc, vc, ks, vs = self.kv_layer(i) if group is None else (None,) * 4
             ws = gemm(y, o + "qkv.w", sp["qkv"])
-            if beam is not None:
+            if group is not None:
+                pre = group["prefix"][i] if group["P"] > 0 else (None, None)
+                G.decode_rope_attention_grouped(ws, pre[0], pre[1], group["row"][i, 0], group["row"][i, 1], d["pos"], self.rope_cos,
+                                                self.rope_sin, 1.0 / math.sqrt(hd), d["a"], group["n"], pdl=pdl)
+            elif beam is not None:
                 G.decode_attention_beam(ws, kc, vc, beam["kv"][i, 0], beam["kv"][i, 1], beam["src"], d["pos"], beam["plen"], self.rope_cos,
                                         self.rope_sin, 1.0 / math.sqrt(hd), d["a"], beam["nb"], pdl=pdl)
             elif hd == 128 and self.fused_rope_attn:

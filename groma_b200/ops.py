@@ -995,6 +995,32 @@ def decode_attention_beam(ws: torch.Tensor, prompt_k: torch.Tensor, prompt_v: to
     return out
 
 
+GROUP_MAX_PROMPTS = 64  # GROMA_GROUP_MAX_PROMPTS: rows of an image in groma_decode_rope_attention_grouped (one wgmma m64 tile)
+
+
+def decode_rope_attention_grouped(ws: torch.Tensor, prefix_k: Optional[torch.Tensor], prefix_v: Optional[torch.Tensor],
+                                  row_k: torch.Tensor, row_v: torch.Tensor, pos_ptr: torch.Tensor, cos_t: torch.Tensor,
+                                  sin_t: torch.Tensor, scale: float, out: torch.Tensor, n: int, pdl: bool = True) -> torch.Tensor:
+    """Decode attention of B images x n prompts with the fused qkv reduce / RoPE / append prologue (include/groma_b200.h:
+    groma_decode_rope_attention_grouped).  ws [S, B*n, 3*H*D] fp32; prefix_k/v [B, H, P, 128] bf16 (None or P = 0: no shared
+    prefix); row_k/v [B*n, H, row_cap, 128] bf16, position p at index p - P; pos_ptr int32 [1]; out bf16 [B*n, H*D]."""
+    S, R, N = ws.shape
+    _, H, rcap, D = row_k.shape
+    B = R // n
+    P = 0 if prefix_k is None else prefix_k.shape[2]
+    assert R == B * n and N == 3 * H * D and tuple(row_k.shape) == (R, H, rcap, D) and tuple(row_v.shape) == (R, H, rcap, D)
+    assert pos_ptr.dtype == torch.int32
+    if P > 0:
+        assert tuple(prefix_k.shape) == (B, H, P, D) and tuple(prefix_v.shape) == (B, H, P, D)
+        assert prefix_k.is_contiguous() and prefix_v.is_contiguous()
+    for t in (ws, row_k, row_v, out):
+        assert t.is_contiguous()
+    _chk(_L().groma_decode_rope_attention_grouped(_p(ws), S, _p(prefix_k) if P > 0 else None, _p(prefix_v) if P > 0 else None, P,
+                                                  _p(row_k), _p(row_v), rcap, _p(pos_ptr), _p(cos_t), _p(sin_t), _p(out), B, n, H, D,
+                                                  float(scale), 1 if pdl else 0, _stream()), "groma_decode_rope_attention_grouped")
+    return out
+
+
 def beam_logsoftmax(logits: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """fp32 log_softmax per row of fp32 logits [rows, V] (include/groma_b200.h: groma_beam_logsoftmax)."""
     _f32(logits, "logits")

@@ -418,6 +418,20 @@ int32_t groma_decode_attention_beam(const float* ws, int32_t splits, const void*
                                     void* beam_k, void* beam_v, int32_t gen_cap, const int32_t* src, const int32_t* pos_ptr,
                                     const int32_t* prompt_len, const float* cos_t, const float* sin_t, void* out, int32_t B,
                                     int32_t nb, int32_t H, int32_t D, float scale, int32_t pdl, void* stream);
+/* ---- prompt groups (generate() with n prompts per image; DESIGN.md sections 3 and 4) ------------------------------------------
+ * groma_decode_rope_attention_grouped: the decode attention of B images x n prompts, rows r = b * n + j, bf16 caches, D = 128,
+ * n <= GROMA_GROUP_MAX_PROMPTS, B * n <= GROMA_BEAM_MAX_ROWS.  prefix_k/v [B, H, prefix_len, 128]: the K/V of the P = prefix_len
+ * positions every row of an image shares, read once per (image, head) and multiplied on the tensor cores (P may be 0).
+ * row_k/v [B * n, H, row_cap, 128]: each row's own positions, position p at index p - P.  Fused prologue as
+ * groma_decode_rope_attention: ws [splits, B * n, 3 * H * 128] are the qkv split-K partials; q and the new K/V row are reduced,
+ * rounded to bf16 and rotated at position *pos_ptr, and the row is stored at row-cache index *pos_ptr - P.  Row r attends to its
+ * image's prefix and its own positions P .. *pos_ptr; the caller keeps P <= *pos_ptr < P + row_cap.  out bf16 [B * n, H * 128].
+ * pdl: programmatic stream serialisation. */
+#define GROMA_GROUP_MAX_PROMPTS 64
+int32_t groma_decode_rope_attention_grouped(const float* ws, int32_t splits, const void* prefix_k, const void* prefix_v,
+                                            int32_t prefix_len, void* row_k, void* row_v, int64_t row_cap, const int32_t* pos_ptr,
+                                            const float* cos_t, const float* sin_t, void* out, int32_t B, int32_t n, int32_t H,
+                                            int32_t D, float scale, int32_t pdl, void* stream);
 /* lp = log_softmax(logits) per row (4.32: `nn.functional.log_softmax(next_token_logits, dim=-1)`): the sum of exp(x - max) and
  * x - (max + log sum) are formed in double in a fixed order, then rounded to fp32. */
 int32_t groma_beam_logsoftmax(const float* logits, int64_t ld, int32_t rows, int32_t V, float* lp, int64_t ld_out, void* stream);
